@@ -14,12 +14,15 @@ A "step" = one pass of the hot path over one batch of synthetic input.  Per rank
 except c4 (strong: one image, files dealt to the ranks).  `value` = work of all ranks / max-over-ranks device time.
   value : inputs and outputs resident in HBM (device-pointer entry points) where the path has one
   e2e   : the reference-facing call with HOST buffers: H2D of the batch and D2H of the results inside the timed region.
-c2 runs with `--inflight` (default 2) steps outstanding through zq_pipe_* -- the counterpart of CompressJob's block
+c2 runs with `--inflight` (default 4) steps outstanding through zq_pipe_* -- the counterpart of CompressJob's block
 queue.  Bracket: barrier + device synchronize, CUDA event, K steps, device synchronize, CUDA event, barrier; max over
 ranks.  `stage_ms` / `roofline` come from a serial pass on ONE context whose stream is torch's current stream, so
-the per-kernel CUDA events there time exactly one kernel each.  Inputs exceed L2 (126 MB) in every config.
+the per-kernel CUDA events there time exactly one kernel each.  Inputs exceed L2 (50 MB on an H100) in every config.
 Parity: every block / digest / fragment table of the timed batch is compared with the reference (oracle/_ref, run once
 on all host cores, outside the timed region) -- config.parity says how many matched.
+--dump-outputs DIR: after the timed steps, what the timed path returned in its last step as DIR/<name>.npy (float32 /
+float64, at most 64 MB; larger arrays as a fixed seeded sample of rows, the row numbers in <name>_rows.npy).  Inputs are
+generated from fixed seeds, so two builds can be compared output for output.
 """
 import argparse
 import hashlib
@@ -63,7 +66,7 @@ def load_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 class ClockSampler(threading.Thread):
@@ -94,6 +97,48 @@ class ClockSampler(threading.Thread):
         reasons = [n for k, n in enumerate(names) if any(len(r) > 2 + k and r[2 + k] == "Active" for r in self.rows)]
         return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": max(mx) if mx else None, "reasons": reasons,
                 "samples": len(self.rows)}
+
+
+def gpu_info(index):
+    """Name, power limit and maximum SM clock of the device: part of every number this script prints."""
+    try:
+        r = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits"],
+                           capture_output=True, text=True, timeout=10)
+        name, plim, mx = [x.strip() for x in r.stdout.strip().split(",")]
+        return {"name": name, "power_limit_w": float(plim), "sm_max_mhz": int(mx)}
+    except Exception:
+        return None
+
+
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(dirpath, arrays):
+    """arrays: name -> integer ndarray (rows along axis 0).  Written as float64 (float32 for byte-valued arrays); an array
+    over its share of DUMP_BYTES is cut to a seeded sample of rows, whose numbers go to <name>_rows.npy."""
+    os.makedirs(dirpath, exist_ok=True)
+    share = DUMP_BYTES // (2 * len(arrays))
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        f = np.float32 if a.dtype == np.uint8 else np.float64
+        row = max(1, a[:1].size) * np.dtype(f).itemsize
+        if a.shape[0] * row > share:
+            rows = np.sort(np.random.default_rng(12345).choice(a.shape[0], share // row, replace=False))
+            np.save(os.path.join(dirpath, name + "_rows.npy"), rows.astype(np.float64))
+            a = a[rows]
+        np.save(os.path.join(dirpath, name + ".npy"), a.astype(f))
+
+
+def block_outputs(out, ooff, olen, prefix=""):
+    """The compressed blocks a caller receives: sizes, offsets, SHA-256 of every block and the bytes of a fixed sample."""
+    n = len(olen)
+    sha = np.zeros((n, 32), dtype=np.uint8)
+    for i in range(n):
+        sha[i] = np.frombuffer(hashlib.sha256(out[int(ooff[i]): int(ooff[i]) + int(olen[i])]).digest(), dtype=np.uint8)
+    pick = np.sort(np.random.default_rng(54321).choice(n, min(n, 16), replace=False))
+    sample = np.concatenate([out[int(ooff[i]): int(ooff[i]) + int(olen[i])] for i in pick]) if n else np.zeros(0, np.uint8)
+    return {prefix + "block_len": olen, prefix + "block_off": ooff, prefix + "block_sha256": sha,
+            prefix + "sample_units": pick, prefix + "sample_bytes": sample}
 
 
 # ---- synthetic workloads (same bytes for both arms) ------------------------------------------------------------
@@ -306,6 +351,8 @@ def main():
     ap.add_argument("--no-parity", action="store_true")
     ap.add_argument("--inflight", type=int, default=4,
                     help="c2: batches in flight (zq_pipe lanes): the next step's copies/kernels fill the tail of the current one")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the timed path returned in its last step to DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -414,6 +461,7 @@ def main():
                 r_ = pipe.wait(t)
                 if world > 1 and not device:
                     exchange(r_[1])
+            state["piped_last"] = ((steps - 1) % depth, r_)
             torch.cuda.synchronize()
             e1.record(stream)
             sync_all()
@@ -426,6 +474,10 @@ def main():
             piped(max(args.warmup, depth), True)
             sampler.start()
             ms_dev, launches = piped(args.steps, True)
+            if args.dump_outputs:
+                lane, (ooff_, olen_) = state["piped_last"]
+                used = int(ooff_[-1]) + int(olen_[-1])
+                dumped = block_outputs(d_outs[lane][:used].cpu().numpy(), ooff_, olen_)
             piped(max(args.warmup, depth), False)
             ms_e2e, _ = piped(args.steps, False)
             d2h_extra = h2d_extra = 0
@@ -438,6 +490,10 @@ def main():
             l0 = ctx.launch_count()
             ms_dev = bracket(step_device, args.steps)
             launches = ctx.launch_count() - l0
+            if args.dump_outputs:
+                ooff_, olen_ = state["dev"]
+                used = int(ooff_[-1]) + int(olen_[-1])
+                dumped = block_outputs(d_outs[0][:used].cpu().numpy(), ooff_, olen_)
             for _ in range(max(1, args.warmup - 1)):
                 step_host()
             ms_e2e = bracket(step_host, args.steps)
@@ -452,6 +508,11 @@ def main():
                 l0 = ctx.launch_count()
                 ms_dec = bracket(step_dec, args.steps)
                 launches += ctx.launch_count() - l0
+                if args.dump_outputs:
+                    dec, doff, dlen = dstate["dec"]
+                    dumped["decoded_len"] = dlen
+                    dumped["decoded_sha256"] = np.stack([np.frombuffer(hashlib.sha256(dec[int(o): int(o) + int(l)]).digest(), dtype=np.uint8)
+                                                         for o, l in zip(doff, dlen)])
                 ms_dev += ms_dec
                 ms_e2e += ms_dec
                 h2d_extra, d2h_extra = int(clen.sum()), nbytes
@@ -504,16 +565,7 @@ def main():
         a_io = nbytes + out_bytes
         algo = a_io + (8 * S_BYTES[method] * coded if method in S_BYTES else 0)
         achieved = algo / 1e9 / (kernels[dom] / 1000) if kernels[dom] > 0 else 0.0
-        traffic, traffic_src = None, None
-        tp = os.path.join(ROOT, "profiles", "traffic_r04.json")
-        if os.path.exists(tp):
-            try:
-                tj = json.load(open(tp))
-                e = tj.get(cfg, {}).get(dom)
-                if e and int(e.get("units", 0)) == U:
-                    traffic, traffic_src = int(e["dram_bytes"]), e.get("source")
-            except Exception:
-                pass
+        traffic, traffic_src = None, None     # DRAM bytes of the kernel: not measured
         line = {
             "metric": metric, "value": round(value, 2), "unit": unit, "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": round(ms_dev / args.steps, 3), "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -523,7 +575,7 @@ def main():
                                       "(zq_dist_exchange_sizes over NCCL, inside the e2e region) -> global archive offsets" if world > 1 else
                                       "one rank: units on one GPU, no collective",
                        "exchanged_bytes_per_rank": zd.bytes_exchanged(),
-                       "l2": "inputs %.0f MB per step > 126 MB L2 (no flush needed)" % (nbytes / MB), "parity": parity,
+                       "l2": "inputs %.0f MB per step > 50 MB L2 (no flush needed)" % (nbytes / MB), "parity": parity,
                        "inflight": depth, "serial_ms_per_step": round(float(st["total"]), 3),
                        "compressed_ratio": round(out_bytes / nbytes, 4)},
             "e2e": {"value": round(e2e_v, 2), "unit": unit, "h2d_bytes_per_step": nbytes + h2d_extra, "d2h_bytes_per_step": out_bytes + d2h_extra,
@@ -538,6 +590,7 @@ def main():
                          "whole_step_frac": round(a_io / 1e9 / (st["total"] / 1000) / peak, 5) if st["total"] > 0 else None,
                          "peak_source": peak_src},
             "clocks": sampler.summary(),
+            "device": gpu_info(local),
         }
         if cfg == "c3":
             line["config"]["note"] = "decompress has no device-pointer entry point: its time is host-to-host in value and e2e alike"
@@ -546,6 +599,8 @@ def main():
                                     "sample": "%d of the %d units (64 KiB each), compress only, all host threads, %.1f s" % (cpu[2], U, cpu[1])}
         if pipe is not None:
             pipe.close()
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, dumped)
     if rank == 0:
         print(json.dumps(line))
     zd.close()
@@ -587,6 +642,8 @@ def run_c4(args, zq, corpus, ctx, zd, ref, rank, world, local, dist, torch, brac
     sampler.stop_flag = True
     sampler.join(timeout=3)
     fl, fh, fs, first = res["frag"]
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"frag_len": fl, "frag_hits": fh, "frag_first": first, "frag_sha1": fs, "file_blake3": res["b3"]})
     # dedup key exchange: 20-byte digests of every rank's fragments -> global unique count (the index the archiver keeps)
     nfrag = len(fl)
     torch.cuda.synchronize()
@@ -639,7 +696,7 @@ def run_c4(args, zq, corpus, ctx, zd, ref, rank, world, local, dist, torch, brac
                                "the ranks longest first" % (total / 1e9, len(sizes)),
                    "files": int(len(sizes)), "image_bytes": int(total), "fragments": tot_frag, "unique_fragments": int(uniq),
                    "parallelism": "files sharded over the ranks; one all-gather of the 20-byte fragment digests (zq_dist_dedup over NCCL: %.1f ms, %d bytes received per rank, outside the step)" % (t_x * 1e3, zd.bytes_exchanged()),
-                   "l2": "inputs %.0f MB per rank per step > 126 MB L2" % (nbytes / MB), "parity": parity,
+                   "l2": "inputs %.0f MB per rank per step > 50 MB L2" % (nbytes / MB), "parity": parity,
                    "note": "host buffers in, tables out: value == e2e (this path has no device-pointer entry point); a file is never split across GPUs"},
         "e2e": {"value": round(value, 3), "unit": "GB/s", "h2d_bytes_per_step": int(2 * nbytes), "d2h_bytes_per_step": int(out_b // world),
                 "ms_per_step": round(ms / args.steps, 3)},
@@ -649,6 +706,7 @@ def run_c4(args, zq, corpus, ctx, zd, ref, rank, world, local, dist, torch, brac
                      "algorithmic_bytes_per_launch": int(2 * total), "algorithmic_bytes_rule": "1.0003 B per input byte for fragmenter + SHA-1, 1 B per byte for BLAKE3; the step includes the H2D copies",
                      "peak_source": peak_src},
         "clocks": sampler.summary(),
+        "device": gpu_info(local),
     }
     if cpu is not None and not args.no_cpu_baseline:
         line["cpu_baseline"] = {"value": round(cpu[0], 3), "unit": "GB/s", "cores": cpu[3], "kind": "reference",

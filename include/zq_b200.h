@@ -1,4 +1,4 @@
-/* zq_b200.h -- C ABI of libzqb200.so: the B200 (sm_100a) implementation of zpaqfranz's two
+/* zq_b200.h -- C ABI of libzqb200.so: the H100 (sm_90a) implementation of zpaqfranz's two
  * data-parallel hot paths (SURVEY.md §8): libzpaq block compression and the dedup fragmenter with
  * its fragment/file hashes.  Plain pointers and sizes only; no C++/torch types cross this line.
  *
@@ -312,7 +312,7 @@ int zq_suffix_array(zq_ctx* ctx, const uint8_t* data, uint32_t n, uint32_t* sa_o
 
 /* CRC-32 (crc32_16bytes, Z:30299: always on in Jidac::updatehash, Z:85948) and XXH64 seed 0 (the archiver's default
  * file hash, XXH64 Z:24688) of n buffers: digests = 4 / 8 bytes per buffer, little-endian.  Bit-exact against zlib and
- * the reference's XXH64 under the emulator and on the B200 (SURVEY.md §8f rank 4). */
+ * the reference's XXH64 under the emulator and on the GPU (SURVEY.md §8f rank 4). */
 int zq_crc32(zq_ctx* ctx, int n, const uint8_t* base, const uint64_t* off, const uint64_t* len, uint8_t* digests);
 int zq_xxh64(zq_ctx* ctx, int n, const uint8_t* base, const uint64_t* off, const uint64_t* len, uint8_t* digests);
 /* MD5 (16 bytes) and SHA3-256 (32 bytes) of n buffers: the -md5 / -sha3 file hashes of updatehash (MD5::add Z:21616,
@@ -325,7 +325,7 @@ int zq_sha3_256(zq_ctx* ctx, int n, const uint8_t* base, const uint64_t* off, co
  * zq_jit_context_source does the source-to-source equivalent for the HCOMP of a block header (hsize ..
  * hcomp 0, as zq_plan_block returns it): a translation unit with `zq_hcomp` (one run of the program) and the
  * kernel `zq_ctx_kernel` (one thread per block, H[0..n) after every byte).  zq_jit_compile runs NVRTC on such a
- * source for sm_100a and reports the cubin size.  Groundwork: the compress path still interprets (DESIGN.md §9).
+ * source for sm_90a and reports the cubin size.  Groundwork: the compress path still interprets (DESIGN.md §9).
  * src may be NULL to query the length.  ZQ_E_UNSUPPORTED: program outside the translator's cover / no NVRTC. */
 int zq_jit_context_source(const uint8_t* header, uint32_t header_len, char* src, uint32_t src_cap, uint32_t* src_len,
                           char* errbuf, size_t errcap);

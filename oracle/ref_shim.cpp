@@ -1,12 +1,12 @@
 // oracle/ref_shim.cpp -- TEST INFRASTRUCTURE ONLY (never linked into the product).
 //
-// Wraps the UNMODIFIED reference translation unit (/root/reference/zpaqfranz.cpp, included by
-// absolute path -- no reference source is copied into this repository) behind a small C ABI so
+// Wraps the UNMODIFIED reference translation unit (zpaqfranz.cpp, found through -I<its directory>: ZPAQFRANZ_SRC
+// names it -- no reference source is copied into this repository) behind a small C ABI so
 // that tests and the bench's CPU-baseline leg can call the reference's own libzpaq::compressBlock,
 // libzpaq::decompress, SHA1/SHA256, XXH3-128, BLAKE3, divsufsort, makeConfig/Compiler and LZBuffer.
-// Built by oracle/Makefile into oracle/_ref/libzpaqref.so (git-ignored; travels to the GPU box).
+// Built by __graft_entry__.build() / oracle/Makefile into oracle/_ref/libzpaqref.so (git-ignored).
 #define main zpaqfranz_reference_main
-#include "/root/reference/zpaqfranz.cpp"
+#include "zpaqfranz.cpp"
 #undef main
 #include <pthread.h>
 #include <atomic>

@@ -3,7 +3,7 @@
  * leg may use it, and only as the checker.
  *
  * A plain-C, single-threaded restatement of the reference's block-compression hot path
- * (/root/reference/zpaqfranz.cpp, "Z:" below), written from the reference's behaviour, not copied:
+ * (zpaqfranz.cpp of fcorbelli/zpaqfranz, "Z:" below), written from the reference's behaviour, not copied:
  *
  *   zqo_sha1              libzpaq::SHA1                       Z:12637-12819
  *   zqo_suffix_array      divsufsort's *result* (the SA is unique)  Z:19121

@@ -12,7 +12,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (select with -m gpu)")
 
 
 def _ensure_built():
@@ -43,11 +43,17 @@ def oracle():
 
 
 @pytest.fixture(scope="session")
-def ref():
-    """oracle/_ref/libzpaqref.so -- the reference itself, compiled from /root/reference (checker)."""
-    _ensure_built()
+def ref(oracle):
+    """The reference's answers (zpaqfranz's own libzpaq): replayed from tests/golden/ref_answers.json.  With
+    ZQ_REF_RECORD=<path> they come from the live reference in oracle/_ref/libzpaqref.so and are written to <path>."""
     import oracle_bindings
-    r = oracle_bindings.load_ref()
-    if r is None:
-        pytest.skip("oracle/_ref/libzpaqref.so not available")
-    return r
+    path = os.environ.get("ZQ_REF_RECORD")
+    if not path:
+        yield oracle_bindings.load_recorded_ref(oracle)
+        return
+    live = oracle_bindings.load_ref()
+    if live is None:
+        pytest.fail("ZQ_REF_RECORD is set but oracle/_ref/libzpaqref.so is not built")
+    r = oracle_bindings.RecordingRef(live)
+    yield r
+    r.save(path)

@@ -1,8 +1,8 @@
 """Generates tests/golden/blocks.json from the REFERENCE itself (oracle/_ref/libzpaqref.so, built from
-/root/reference by oracle/Makefile): for small deterministic inputs and a spread of methods, the exact
-bytes libzpaq::compressBlock writes, plus reference digests.  Run in the build container:
+the reference's zpaqfranz.cpp by oracle/Makefile): for small deterministic inputs and a spread of methods, the exact
+bytes libzpaq::compressBlock writes, plus reference digests.  Run where oracle/_ref/libzpaqref.so is built:
     python tests/golden/make_golden.py
-The fixtures let the parity tests run where neither /root/reference nor the prebuilt _ref exists."""
+The fixtures let the parity tests run where neither the reference nor the prebuilt _ref exists."""
 import base64
 import json
 import os

@@ -1,6 +1,6 @@
 """Generates tests/golden/sha256_zpaq.json: what the REFERENCE's own decoder (oracle/_ref) makes of every block of the
 decoder fixture the reference ships, AUTOTEST/sha256.zpaq (copied verbatim to tests/golden/sha256.zpaq; -m5, 256 files
-of 37 000 bytes named by the SHA-256 of their content, AUTOTEST/README.txt:1-45).  Run in the build container:
+of 37 000 bytes named by the SHA-256 of their content, AUTOTEST/README.txt:1-45).  Run where oracle/_ref/libzpaqref.so is built:
     python tests/golden/make_golden_archive.py"""
 import hashlib
 import json

@@ -183,7 +183,7 @@ def test_cpp_caller_of_the_c_abi(zq, oracle, tmp_path):
 @pytest.mark.gpu
 @pytest.mark.parametrize("kind,world", [("mixed", 3), ("zeros_at_cut", 2)])
 def test_device_fragmenter_pieces_equal_the_whole_stream(ctx, oracle, kind, world):
-    """Every piece through zq_fragment on the B200 (fragment 6, the archiver's default): lengths and SHA-1s of the
+    """Every piece through zq_fragment on the GPU (fragment 6, the archiver's default): lengths and SHA-1s of the
     kept fragments equal those of one zq_fragment call over the whole stream and the oracle's lengths."""
     fragment = 6
     data = _stream(kind, 24_000_000)

@@ -1,5 +1,5 @@
 """Committed golden vectors (tests/golden/blocks.json, produced by the reference through
-tests/golden/make_golden.py): the plain-C oracle on CPU, and the CUDA path on the GPU box, must reproduce
+tests/golden/make_golden.py): the plain-C oracle on CPU, and the CUDA path on the GPU, must reproduce
 them byte for byte even where the reference itself is not available."""
 import base64
 import json

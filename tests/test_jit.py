@@ -1,6 +1,6 @@
 """ZPAQL -> CUDA C translation (zpaqfranz_b200/csrc/zq_jit.cpp): the generated code, compiled for the host, is stepped
 against the device interpreter over the same bytes (registers, H, R, M must agree after every byte), and NVRTC compiles
-the generated translation unit for sm_100a.  No GPU needed; the compress path does not use the translator yet."""
+the generated translation unit for sm_90a.  No GPU needed; the compress path does not use the translator yet."""
 import ctypes as C
 import os
 import subprocess
@@ -110,7 +110,7 @@ CODER_MODELS = ["method 36,200,1", "method 3", "method 4", "method 5", "method 4
 @pytest.mark.parametrize("name", CODER_MODELS)
 def test_generated_model_codes_like_the_oracle(name, oracle, tmp_path):
     """The model written out as straight-line code (zq_encode_block) + the translated context program, compiled for the
-    host: coded bytes equal the oracle's; NVRTC compiles the same translation unit for sm_100a."""
+    host: coded bytes equal the oracle's; NVRTC compiles the same translation unit for sm_90a."""
     from test_cm_emu import _coded_by_oracle
     header = HEADERS[name]()
     src = _coder_source(header)

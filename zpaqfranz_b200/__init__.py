@@ -1,4 +1,4 @@
-"""zpaqfranz_b200 -- B200-native (sm_100a) implementation of zpaqfranz's block compressor and dedup
+"""zpaqfranz_b200 -- H100-native (sm_90a) implementation of zpaqfranz's block compressor and dedup
 fragmenter hot paths, behind the reference's libzpaq API.
 
 This package is a thin ctypes view of the C-ABI shared library (include/zq_b200.h).  The compute is

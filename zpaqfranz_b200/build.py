@@ -1,7 +1,7 @@
-"""Builds libzqb200.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Builds libzqb200.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
 Usage: python zpaqfranz_b200/build.py [--force] [-v]   (run by path: the package itself needs the library)
-The built .so is git-ignored but travels to the GPU box with the gpurun snapshot.
+The built .so is git-ignored; it is rebuilt when a source, a header or this file (the flags) is newer.
 """
 import os
 import subprocess
@@ -12,7 +12,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.environ.get("ZQ_LIB", os.path.join(HERE, "libzqb200.so"))   # ZQ_LIB: a tuning build beside the shipped one
 SOURCES = ["zq_api.cu", "zq_config.cpp", "zq_cm_host.cpp", "libzpaq_b200.cpp", "zq_archive.cpp", "zq_pipe.cpp", "zq_jit.cpp", "zq_dist.cpp"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-Wall", "-shared", "-cudart", "static",
 ]
 
@@ -21,6 +21,8 @@ def _stale():
     if not os.path.exists(LIB):
         return True
     t = os.path.getmtime(LIB)
+    if os.path.getmtime(os.path.abspath(__file__)) > t:
+        return True
     for root in (CSRC, os.path.join(HERE, "..", "include")):
         for f in os.listdir(root):
             if os.path.getmtime(os.path.join(root, f)) > t:

@@ -72,9 +72,9 @@ struct zq_ctx {
   bool attr_cm_enc = false, attr_cm_dec = false, attr_sort16 = false;
   int sort16 = 1;                         // blocks <= 64 KiB: shared-memory sort (zq_sufsort16.cuh); ZQ_SORT16=0 sends everything to k_suffix_sort
   float last_ms[16] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-  size_t wave_bytes = (size_t)24 << 30;  // sa|isa|lcp|bwt|scan-table bytes per wave
+  size_t wave_bytes = 0;                 // sa|isa|lcp|bwt|scan-table bytes per wave (zq_create: 1/16 of device memory)
   size_t model_budget = (size_t)120 << 30; // component-table bytes per wave (capped by free memory)
-  int sort_nt = 256, sort_minb = 4;       // suffix-sort CTA size and CTAs per SM (measured best: 95.9 ms vs 103.5 ms at 512x2)
+  int sort_nt = 256, sort_minb = 4;       // suffix-sort CTA size and CTAs per SM (ZQ_SORT_NT / ZQ_SORT_MINB select the others)
   uint64_t frag_seg = 128 << 10;          // fragmenter segment size
   int lz_old = 0;                         // 1: warp-per-block LZ77 parser for every block (ZQ_LZ_OLD=1); 0: position-parallel scan/walk/emit (zq_lz77_scan.cuh)
   int scan_occ[2][2] = {{0, 0}, {0, 0}};  // resident CTAs per SM of k_lz_scan<u16/u32, pass> (queried once)
@@ -305,6 +305,7 @@ int compress_core(zq_ctx* c, int n, const uint8_t* d_in, const uint64_t* in_off,
   gate.acquire();
   std::vector<uint32_t> lz_len_h(n, 0), coded_len_h(n, 0);
   uint64_t out_pos = 0;
+  float stage_ms[16] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};   // per stage, summed over the waves
   int w0 = 0;
   while (w0 < n) {
     size_t work = 0, lzbytes = 0, maxn = 0, model = 0, coded = 0, htbytes = 0;
@@ -567,8 +568,8 @@ int compress_core(zq_ctx* c, int n, const uint8_t* d_in, const uint64_t* in_off,
         uint64_t ctx_elems = 0;
         for (auto& g : groups) {
           const ZqCmPlan& cp = cmplans[g.first];
-          // measured on B200: -m3 (2 components) 442 -> 294 ms per 100 MB with the translated program, -m5 (22) 10 % slower
-          // (its coder is the critical path and the context table of every byte costs traffic)
+          // the translated program pays off for small models (-m3, 2 components); -m5 (22) is slower with it: its coder is
+          // the critical path and the context table of every byte costs traffic
           if (c->cm_jit_auto && cp.n > 8) continue;
           if (cp.n > ZQ_CM_LANES) continue;                                // wide models: one lane does everything (zq_cm_wide.cuh)
           const u8* hc = blob.data() + cp.hcomp_off;
@@ -695,6 +696,11 @@ int compress_core(zq_ctx* c, int n, const uint8_t* d_in, const uint64_t* in_off,
     ++c->launches;
     tstop(c, 4);
     ZQ_CUDA(c, cudaStreamSynchronize(c->stream));  // host vectors of this wave go out of scope
+    for (int k = 1; k < 16; ++k) {
+      float ms = 0;
+      if (c->tm[k].used && cudaEventElapsedTime(&ms, c->tm[k].a, c->tm[k].b) == cudaSuccess) stage_ms[k] += ms;
+      c->tm[k].used = false;
+    }
     w0 = w1;
   }
   tstop(c, 0);
@@ -704,10 +710,9 @@ int compress_core(zq_ctx* c, int n, const uint8_t* d_in, const uint64_t* in_off,
   ZQ_CUDA(c, cudaGetLastError());
   if (errflag & 2) return fail(c, ZQ_E_METHOD, "ZPAQL execution error");
   if (errflag) return fail(c, ZQ_E_OUTPUT, "internal: intermediate stream exceeded its bound");
-  for (int k = 0; k < 16; ++k) {
-    c->last_ms[k] = 0;
-    if (c->tm[k].used) cudaEventElapsedTime(&c->last_ms[k], c->tm[k].a, c->tm[k].b);
-  }
+  c->last_ms[0] = 0;
+  cudaEventElapsedTime(&c->last_ms[0], c->tm[0].a, c->tm[0].b);
+  for (int k = 1; k < 16; ++k) c->last_ms[k] = stage_ms[k];
   return ZQ_OK;
 }
 
@@ -751,7 +756,7 @@ static int hash_many(zq_ctx* c, int n, const uint8_t* base, const uint64_t* off,
 // =================================================================================================
 extern "C" {
 
-const char* zq_version(void) { return "zpaqfranz_b200 0.1 (sm_100a)"; }
+const char* zq_version(void) { return "zpaqfranz_b200 0.1 (sm_90a)"; }
 
 zq_ctx* zq_create(int device) {
   int ndev = 0;
@@ -767,6 +772,9 @@ zq_ctx* zq_create(int device) {
   cudaDeviceProp prop;
   cudaGetDeviceProperties(&prop, device);
   c->num_sms = prop.multiProcessorCount;
+  // a wave's scratch (work tables, tokens, LZ streams) comes to ~1.6x wave_bytes; 1/16 of the device keeps the four
+  // contexts of a zq_pipe of depth 4 within 40 % of an 80 GB H100 (5 GB: ~3 400 blocks of 64 KiB per wave)
+  c->wave_bytes = std::max<size_t>(prop.totalGlobalMem / 16, (size_t)64 << 20);
   if (cudaStreamCreateWithFlags(&c->own_stream, cudaStreamNonBlocking) != cudaSuccess) { g_create_error = "stream creation failed"; delete c; return nullptr; }
   c->stream = c->own_stream;
   for (int k = 0; k < 16; ++k) { cudaEventCreate(&c->tm[k].a); cudaEventCreate(&c->tm[k].b); }

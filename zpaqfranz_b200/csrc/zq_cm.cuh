@@ -225,8 +225,8 @@ __device__ void cm_vm_run_switch(CmVm& v, u32 input, VmOut* o) {
 }
 #undef ZQ_VM_X8
 
-// (two branch-free forms of this interpreter -- arithmetic selects, with and without predicated loads -- were measured
-//  slower on B200: 355 / 262 ms vs 236 ms per 100 MB of BWT blocks, profiles/README.md r01l, r01m -- and removed)
+// (two branch-free forms of this interpreter -- arithmetic selects, with and without predicated loads -- were slower
+//  than the switch on BWT blocks and were removed)
 template <int VM, bool WITH_OUT>
 __device__ __forceinline__ void cm_vm_run(CmVm& v, u32 input, VmOut* o) { cm_vm_run_switch<WITH_OUT>(v, input, o); }
 
@@ -687,7 +687,7 @@ __global__ void k_ctx_args(const ZqUnit* __restrict__ units, const ZqPlan* __res
 
 // grid of persistent CTAs of `blockDim.x / 64` warp pairs (even warp: coder, odd warp: context machine);
 // pairs pull modeled units from a counter.  Dynamic shared memory: CmSmem + one CmUnitSmem per pair.
-#define ZQ_CM_MAX_PAIRS 12   // 768 threads: 85 registers per thread without spills; 1 776 blocks resident on 148 SMs
+#define ZQ_CM_MAX_PAIRS 12   // 768 threads: 80 registers per thread (sm_90a: 44 bytes spilled); 1 584 blocks resident on 132 SMs
 template <int VM, bool CTX>   // CTX: contexts of some blocks arrive precomputed (translated HCOMP, zq_jit.cpp)
 __global__ void __launch_bounds__(64 * ZQ_CM_MAX_PAIRS, 1)
 k_cm_encode(const u8* __restrict__ in_base, const ZqUnit* __restrict__ units, const ZqPlan* __restrict__ plans,

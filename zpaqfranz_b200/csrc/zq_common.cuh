@@ -1,4 +1,4 @@
-// zq_common.cuh -- shared device helpers and descriptors for the sm_100a kernels.
+// zq_common.cuh -- shared device helpers and descriptors for the sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -2,7 +2,7 @@
 // the ZPAQL assembler. Everything here is tiny, runs once per (method, block size) and only has to
 // produce the exact header / PCOMP bytes the reference would write (SURVEY.md §8 a1-a3).
 //
-// Reference behaviour restated (not copied) from /root/reference/zpaqfranz.cpp:
+// Reference behaviour restated (not copied) from the reference's zpaqfranz.cpp:
 //   compressBlock digit-level table  Z:20289-20390
 //   makeConfig                       Z:19615-20247
 //   Compiler (ZPAQL assembler)       Z:15602-15969

@@ -8,7 +8,7 @@
 // (as four 256-entry tables built on the host) -- the same algebra as the reference's crc32_combine (Z:30382).
 // XXH64 is a sequential recurrence over 32-byte stripes: one thread per buffer.
 // Checked bit for bit against zlib and the reference's own XXH64 under the SIMT emulator (tests/test_hash_emu.py) and on
-// the B200 (tests/test_gpu_hashes.py).
+// the GPU (tests/test_gpu_hashes.py).
 #pragma once
 #include "zq_common.cuh"
 

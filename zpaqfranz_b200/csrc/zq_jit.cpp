@@ -178,7 +178,7 @@ int jit_compile(const std::string& src, std::vector<char>& cubin, std::string& l
   if (!create || !compile || !logsize || !getlog || !binsize || !getbin || !destroy) { log = "libnvrtc lacks the expected entry points"; return -1; }
   void* prog = nullptr;
   if (create(&prog, src.c_str(), "zq_jit.cu", 0, nullptr, nullptr) != 0) { log = "nvrtcCreateProgram failed"; return -2; }
-  const char* opts[] = {"--gpu-architecture=sm_100a", "-lineinfo", "--std=c++17"};
+  const char* opts[] = {"--gpu-architecture=sm_90a", "-lineinfo", "--std=c++17"};
   const int rc = compile(prog, 3, opts);
   size_t ls = 0;
   if (logsize(prog, &ls) == 0 && ls > 1) { log.resize(ls); getlog(prog, &log[0]); }

@@ -3,12 +3,12 @@
 // The reference does not interpret ZPAQL on its hot path either: libzpaq translates HCOMP/PCOMP to x86 machine code
 // when a block starts (ZPAQL::assemble, Z:16358, called from ZPAQL::run Z:17677; interpreter only under `flagnojit`).  The device counterpart is
 // source-to-source: one labelled C statement per ZPAQL instruction, jumps become gotos, M/H sizes are baked in as
-// constants, then NVRTC -> cubin for sm_100a.  ncu (profiles/r01j) has the interpreted context machine as the critical
+// constants, then NVRTC -> cubin for sm_90a.  ncu (profiles/r01j) has the interpreted context machine as the critical
 // path of the chain models (~380 cycles per ZPAQL instruction against a handful of SASS instructions translated).
 //
 // Status: on the compress path (zq_api.cu loads the module per model, cached; default for models of <= 8 components,
 // ZQ_CM_JIT forces a form).  The CPU tests compile the generated code for the host and step it against the
-// interpreter, NVRTC compiles it for sm_100a without a GPU, the GPU tests run all three forms bit for bit
+// interpreter, NVRTC compiles it for sm_90a without a GPU, the GPU tests run all three forms bit for bit
 // (tests/test_gpu_compress.py::test_context_program_forms_over_several_waves).
 #pragma once
 #include <cstdint>
@@ -34,7 +34,7 @@ bool jit_context_source(const uint8_t* hcomp, size_t len, int hh, int hm, int nc
 struct ZqCmPlanRef;   // (ZqCmPlan from zq_cm_types.h; declared in the .cpp to keep this header light)
 bool jit_coder_source(const void* zq_cm_plan, std::string& src, std::string& why);
 
-// NVRTC (dlopen'ed, no link-time dependency): source -> cubin for sm_100a.  Returns 0 or a negative code with `log`.
+// NVRTC (dlopen'ed, no link-time dependency): source -> cubin for sm_90a.  Returns 0 or a negative code with `log`.
 int jit_compile(const std::string& src, std::vector<char>& cubin, std::string& log);
 
 }  // namespace zq
